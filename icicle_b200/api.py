@@ -12,7 +12,7 @@ import enum
 import numpy as np
 
 from . import capi
-from .capi import IcicleError, MsmConfigC, NttConfigC, VecOpsConfigC, lib, check
+from .capi import IcicleError, MatMulConfigC, MsmConfigC, NttConfigC, VecOpsConfigC, lib, check
 
 
 class Field(enum.IntEnum):
@@ -615,6 +615,52 @@ def matrix_transpose(field, a, rows, cols, config=None, output=None):
     cfg = config or VecOpsConfig()
     fn, ap, op, c, output = _unary("b200_matrix_transpose", field, a, rows * cols * cfg.batch_size, field_limbs(field), cfg, output)
     check(fn(int(field), ap, int(rows), int(cols), C.byref(c), op), "matrix_transpose")
+    return output
+
+
+class MatMulConfig:
+    """icicle::MatMulConfig (icicle/include/icicle/mat_ops.h:20-30)."""
+
+    def __init__(self, **kw):
+        self.stream = None
+        self.is_a_on_device = False
+        self.is_b_on_device = False
+        self.is_result_on_device = False
+        self.a_transposed = False
+        self.b_transposed = False
+        self.result_transposed = False
+        self.is_async = False
+        for k, v in kw.items():
+            if not hasattr(self, k):
+                raise TypeError(f"MatMulConfig has no field {k}")
+            setattr(self, k, v)
+
+    def _c(self):
+        c = MatMulConfigC()
+        lib.b200_matmul_default_config(C.byref(c))
+        c.stream = _stream_handle(self.stream)
+        for name in ("is_a_on_device", "is_b_on_device", "is_result_on_device", "a_transposed", "b_transposed", "result_transposed",
+                     "is_async"):
+            setattr(c, name, 1 if getattr(self, name) else 0)
+        return c
+
+
+def matmul(field, a, rows_a, cols_a, b, rows_b, cols_b, config=None, output=None):
+    """out = op(A) x op(B) (icicle/src/matrix_ops.cpp:8-37): row-major, standard form; op(X) = X^T when the config's
+    a_transposed / b_transposed is set.  Returns output, (eff_rows_a * eff_cols_b, limbs), on the device when
+    config.is_result_on_device."""
+    cfg = copy.copy(config) if config else MatMulConfig()
+    ap, a_dev, _ka = _ptr(a)
+    bp, b_dev, _kb = _ptr(b)
+    cfg.is_a_on_device, cfg.is_b_on_device = a_dev, b_dev
+    if output is None:
+        rows = cols_a if cfg.a_transposed else rows_a
+        cols = rows_b if cfg.b_transposed else cols_b
+        output = _out_like(field, rows * cols, cfg.is_result_on_device)
+    op, o_dev, _ko = _out_ptr(output)
+    cfg.is_result_on_device = o_dev
+    c = cfg._c()
+    check(lib.b200_matmul(int(field), ap, int(rows_a), int(cols_a), bp, int(rows_b), int(cols_b), C.byref(c), op), "matmul")
     return output
 
 

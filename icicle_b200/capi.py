@@ -49,6 +49,14 @@ class VecOpsConfigC(C.Structure):
     ]
 
 
+class MatMulConfigC(C.Structure):
+    _fields_ = [
+        ("stream", C.c_void_p), ("is_a_on_device", C.c_uint8), ("is_b_on_device", C.c_uint8), ("is_result_on_device", C.c_uint8),
+        ("a_transposed", C.c_uint8), ("b_transposed", C.c_uint8), ("result_transposed", C.c_uint8), ("is_async", C.c_uint8),
+        ("reserved", C.c_uint8),
+    ]
+
+
 # every symbol include/icicle_b200.h declares: name -> (restype, argtypes)
 _vp, _i, _u64, _u32, _sz = C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.c_size_t
 SYMBOLS = {
@@ -100,6 +108,8 @@ SYMBOLS = {
     "b200_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),
     "b200_bit_reverse": (_i, [_i, _vp, _u64, C.POINTER(VecOpsConfigC), _vp]),
     "b200_matrix_transpose": (_i, [_i, _vp, _u32, _u32, C.POINTER(VecOpsConfigC), _vp]),
+    "b200_matmul_default_config": (None, [C.POINTER(MatMulConfigC)]),
+    "b200_matmul": (_i, [_i, _vp, _u32, _u32, _vp, _u32, _u32, C.POINTER(MatMulConfigC), _vp]),
     "b200_slice": (_i, [_i, _vp, _u64, _u64, _u64, _u64, C.POINTER(VecOpsConfigC), _vp]),
     "b200_affine_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),
     "b200_projective_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),

@@ -247,6 +247,28 @@ B200_API int b200_convert_montgomery(int field, const void* in, uint64_t size, i
 B200_API int b200_bit_reverse(int field, const void* in, uint64_t size, const b200_vec_ops_config* cfg, void* out);
 /* matrix_transpose (vec_ops_backend.h:204-212; cpu_matrix_ops.cpp): out[c*rows + r] = in[r*cols + c] */
 B200_API int b200_matrix_transpose(int field, const void* in, uint32_t rows, uint32_t cols, const b200_vec_ops_config* cfg, void* out);
+/* matmul -- replaces the scalarBinaryMatrixOpImpl hook (REGISTER_MATMUL_BACKEND, icicle/include/icicle/backend/mat_ops_backend.h:11-31;
+ * frontend <prefix>_matmul, icicle/src/matrix_ops.cpp:8-37), i.e. cpu_matmul<scalar_t> (icicle/backend/cpu/src/field/
+ * cpu_matrix_ops.cpp:44-123,367).  Mirror of icicle::MatMulConfig (icicle/include/icicle/mat_ops.h:20-30).
+ * out = op(A) x op(B), row-major, standard form; op(A) = A^T when a_transposed (element (r,k) = a[k*cols_a + r]), op(B) = B^T
+ * when b_transposed (element (k,c) = b[c*cols_b + k]); out is eff_rows_a x eff_cols_b.  INVALID_ARGUMENT for a null matrix,
+ * a zero dimension, result_transposed (unsupported by the reference, cpu_matrix_ops.cpp:58-68) or mismatched inner
+ * dimensions; the base-field ids only (the *_EXT4 ids give API_NOT_IMPLEMENTED, like the reference's scalar_t-only hook). */
+typedef struct {
+  void* stream;
+  uint8_t is_a_on_device;
+  uint8_t is_b_on_device;
+  uint8_t is_result_on_device;
+  uint8_t a_transposed;
+  uint8_t b_transposed;
+  uint8_t result_transposed;
+  uint8_t is_async;
+  uint8_t reserved;
+} b200_matmul_config;
+
+B200_API void b200_matmul_default_config(b200_matmul_config* cfg);     /* default_mat_mul_config(), mat_ops.h:37 */
+B200_API int b200_matmul(int field, const void* a, uint32_t rows_a, uint32_t cols_a, const void* b, uint32_t rows_b, uint32_t cols_b,
+                         const b200_matmul_config* cfg, void* out);
 /* slice (cpu_vec_ops.cpp:577-596): out[i] = in[offset + i*stride] */
 B200_API int b200_slice(int field, const void* in, uint64_t offset, uint64_t stride, uint64_t size_in, uint64_t size_out,
                const b200_vec_ops_config* cfg, void* out);
