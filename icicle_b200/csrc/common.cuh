@@ -10,6 +10,7 @@
 #include "ext.cuh"
 #include "ext4.cuh"
 #include "goldilocks.cuh"
+#include "ext2.cuh"
 #include "ec.cuh"
 
 namespace b200 {
@@ -192,6 +193,10 @@ static inline int num_sms()
     B200_FIELD_CASE(B200_FIELD_GOLDILOCKS, goldilocks, __VA_ARGS__)                                                    \
     B200_EXT4_CASE(B200_FIELD_BABYBEAR_EXT4, babybear, __VA_ARGS__)                                                    \
     B200_EXT4_CASE(B200_FIELD_KOALABEAR_EXT4, koalabear, __VA_ARGS__)                                                  \
+  case B200_FIELD_GOLDILOCKS_EXT2: {                                                                                   \
+    using F = ::b200::Ext2;                                                                                            \
+    __VA_ARGS__;                                                                                                       \
+  } break;                                                                                                             \
   default:                                                                                                             \
     return B200_INVALID_ARGUMENT;                                                                                      \
   }
@@ -220,7 +225,7 @@ static inline int field_limbs(int field)
   case B200_FIELD_BW6_761_FQ: return 24;
   case B200_FIELD_BABYBEAR: case B200_FIELD_KOALABEAR: case B200_FIELD_M31: return 1;
   case B200_FIELD_GOLDILOCKS: return 2;
-  case B200_FIELD_BABYBEAR_EXT4: case B200_FIELD_KOALABEAR_EXT4: return 4;
+  case B200_FIELD_BABYBEAR_EXT4: case B200_FIELD_KOALABEAR_EXT4: case B200_FIELD_GOLDILOCKS_EXT2: return 4;
   default: return 0;
   }
 }

@@ -264,13 +264,14 @@ int b200_matmul(int field, const void* a, uint32_t rows_a, uint32_t cols_a, cons
                 const b200_matmul_config* cfg, void* out)
 {
   if (!cfg) return B200_INVALID_POINTER;
-  if (field == B200_FIELD_BABYBEAR_EXT4 || field == B200_FIELD_KOALABEAR_EXT4) return B200_API_NOT_IMPLEMENTED; // scalar_t only
+  if (field == B200_FIELD_BABYBEAR_EXT4 || field == B200_FIELD_KOALABEAR_EXT4 || field == B200_FIELD_GOLDILOCKS_EXT2)
+    return B200_API_NOT_IMPLEMENTED; // scalar_t only
   // argument checks in the reference's order (cpu_matrix_ops.cpp:55-76)
   if (!a || !b || !out || rows_a == 0 || cols_a == 0 || rows_b == 0 || cols_b == 0) return B200_INVALID_ARGUMENT;
   if (cfg->result_transposed) return B200_INVALID_ARGUMENT;
   if ((cfg->a_transposed ? rows_a : cols_a) != (cfg->b_transposed ? cols_b : rows_b)) return B200_INVALID_ARGUMENT;
 #define B200_MM_CASE(ID, PARAMS) B200_FIELD_CASE(ID, PARAMS, return matmul_impl<F>(a, rows_a, cols_a, b, rows_b, cols_b, cfg, out))
-  switch (field) { // B200_DISPATCH_FIELD without the EXT4 ids
+  switch (field) { // B200_DISPATCH_FIELD without the extension ids
     B200_MM_CASE(B200_FIELD_BN254_FR, bn254_fr)
     B200_MM_CASE(B200_FIELD_BN254_FQ, bn254_fq)
     B200_MM_CASE(B200_FIELD_BLS12_381_FR, bls12_381_fr)

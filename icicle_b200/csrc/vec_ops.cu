@@ -120,21 +120,21 @@ __global__ void __launch_bounds__(VEC_THREADS) k_slice(
   }
 }
 
-// extension_vector_mixed_mul: out[i] = a[i] (quartic extension) * b[i] (base field), standard form in and out
-template <class P>
+// extension_vector_mixed_mul: out[i] = a[i] (extension E) * b[i] (its base field E::B), standard form in and out
+template <class E>
 __global__ void __launch_bounds__(VEC_THREADS) k_ext_mixed_mul(const uint32_t* __restrict__ a, const uint32_t* __restrict__ b, uint32_t* out, uint64_t n)
 {
-  typedef Ext4<P> E;
-  typedef Fp<P> B;
+  typedef typename E::B B;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const E x = load_fp<E>(a + i * 4);
-    const B y = load_fp<B>(b + i).to_mont(); // (x_c * yR) / R = x_c * y
-    store_fp<E>(out + i * 4, x.scale(y));
+    const E x = load_fp<E>(a + i * E::N);
+    const B y = load_fp<B>(b + i * B::N).to_mont(); // (x_c * yR) / R = x_c * y
+    store_fp<E>(out + i * E::N, x.scale(y));
   }
 }
-template <class P>
+template <class E>
 int ext_mixed_mul_impl(const void* a, const void* b, uint64_t size, const b200_vec_ops_config* cfg, void* out)
 {
+  typedef typename E::B B;
   cudaStream_t s = (cudaStream_t)cfg->stream;
   const uint64_t n = size * (cfg->batch_size > 0 ? cfg->batch_size : 1);
   if (n == 0) return B200_SUCCESS;
@@ -142,12 +142,12 @@ int ext_mixed_mul_impl(const void* a, const void* b, uint64_t size, const b200_v
   const void *da, *db;
   void* dout;
   int err;
-  if ((err = stage_in(da, a, n * 16, cfg->is_a_on_device, s, sa))) return err;
-  if ((err = stage_in(db, b, n * 4, cfg->is_b_on_device, s, sb))) return err;
-  if ((err = stage_out(dout, out, n * 16, cfg->is_result_on_device, s, so))) return err;
-  k_ext_mixed_mul<P><<<grid_for(n), VEC_THREADS, 0, s>>>((const uint32_t*)da, (const uint32_t*)db, (uint32_t*)dout, n); B200_LAUNCHED(1);
+  if ((err = stage_in(da, a, n * E::BYTES, cfg->is_a_on_device, s, sa))) return err;
+  if ((err = stage_in(db, b, n * B::BYTES, cfg->is_b_on_device, s, sb))) return err;
+  if ((err = stage_out(dout, out, n * E::BYTES, cfg->is_result_on_device, s, so))) return err;
+  k_ext_mixed_mul<E><<<grid_for(n), VEC_THREADS, 0, s>>>((const uint32_t*)da, (const uint32_t*)db, (uint32_t*)dout, n); B200_LAUNCHED(1);
   B200_CUDA_TRY(cudaGetLastError(), B200_UNKNOWN_ERROR);
-  return finish_out(out, dout, n * 16, cfg->is_result_on_device, cfg->is_async, s);
+  return finish_out(out, dout, n * E::BYTES, cfg->is_result_on_device, cfg->is_async, s);
 }
 
 template <class F>
@@ -577,8 +577,9 @@ int b200_vec_op(int field, int op, const void* a, const void* b, uint64_t size, 
 int b200_ext_mixed_mul(int ext_field, const void* a, const void* b, uint64_t size, const b200_vec_ops_config* cfg, void* out)
 {
   if (!cfg || !a || !b || !out) return B200_INVALID_POINTER;
-  if (ext_field == B200_FIELD_BABYBEAR_EXT4) return ext_mixed_mul_impl<params::babybear>(a, b, size, cfg, out);
-  if (ext_field == B200_FIELD_KOALABEAR_EXT4) return ext_mixed_mul_impl<params::koalabear>(a, b, size, cfg, out);
+  if (ext_field == B200_FIELD_BABYBEAR_EXT4) return ext_mixed_mul_impl<Ext4<params::babybear>>(a, b, size, cfg, out);
+  if (ext_field == B200_FIELD_KOALABEAR_EXT4) return ext_mixed_mul_impl<Ext4<params::koalabear>>(a, b, size, cfg, out);
+  if (ext_field == B200_FIELD_GOLDILOCKS_EXT2) return ext_mixed_mul_impl<Ext2>(a, b, size, cfg, out);
   return B200_INVALID_ARGUMENT;
 }
 
@@ -642,6 +643,12 @@ int b200_convert_montgomery(int field, const void* in, uint64_t size, int is_int
     c.is_b_on_device = cfg->is_a_on_device;
     c.is_a_on_device = 0; // the scalar lives on the host
     return b200_vec_op(field, B200_SCALAR_MUL_VEC, k.v, in, n, &c, out);
+  }
+  if (field == B200_FIELD_GOLDILOCKS_EXT2) { // coefficient-wise (goldilocks.h:411-419): the Goldilocks conversion over 2n values
+    b200_vec_ops_config c = *cfg;
+    c.batch_size = 1;
+    c.columns_batch = 0;
+    return b200_convert_montgomery(B200_FIELD_GOLDILOCKS, in, 2 * n, is_into, &c, out);
   }
   if (field == B200_FIELD_M31) { // the reference's MersenneField: to/from_montgomery are the identity (m31.h:232-234)
     cudaStream_t s = (cudaStream_t)cfg->stream;

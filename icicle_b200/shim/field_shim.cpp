@@ -128,11 +128,13 @@ namespace {
     return to_err(b200_matmul(FIELD, a, rows_a, cols_a, b, rows_b, cols_b, &c, out));
   }
 
-#if defined(EXT_FIELD) && (FIELD_ID == BABY_BEAR || FIELD_ID == KOALA_BEAR)
-  #define B200_HAS_EXT4 1
+#if defined(EXT_FIELD) && (FIELD_ID == BABY_BEAR || FIELD_ID == KOALA_BEAR || FIELD_ID == GOLDILOCKS)
+  #define B200_HAS_EXT 1
   // REGISTER_*_EXT_FIELD_BACKEND family (vec_ops_backend.h:297-494): the same C-ABI entry points with the extension's field id
   constexpr int EXT = ext_field_id();
-  static_assert(sizeof(extension_t) == 4 * sizeof(scalar_t), "quartic extension");
+  static_assert(EXT >= 0, "no device extension field for this build");
+  static_assert(sizeof(extension_t) == 16 && (sizeof(extension_t) == 4 * sizeof(scalar_t) || sizeof(extension_t) == 2 * sizeof(scalar_t)),
+                "16-byte extension of 2 or 4 base-field coefficients");
   template <int OP>
   eIcicleError ext_vec2(const Device&, const extension_t* a, const extension_t* b, uint64_t size, const VecOpsConfig& config, extension_t* out)
   {
@@ -222,7 +224,8 @@ namespace {
   // NttExtFieldImpl (ntt_backend.h:32-48): extension_t elements, scalar_t twiddles / coset generator / domain
   eIcicleError ntt_ext_impl(const Device&, const extension_t* in, int size, NTTDir dir, const NTTConfig<scalar_t>& config, extension_t* out)
   {
-    static_assert(sizeof(extension_t) == 4 * sizeof(scalar_t), "b200_ntt_extension implements the quartic extension");
+    static_assert(sizeof(extension_t) == 16 && (sizeof(extension_t) == 4 * sizeof(scalar_t) || sizeof(extension_t) == 2 * sizeof(scalar_t)),
+                  "b200_ntt_extension implements 16-byte extensions of 2 or 4 base-field coefficients");
     b200_ntt_config c = to_c(config);
     return to_err(b200_ntt_extension(FIELD, in, size, dir == NTTDir::kForward ? B200_NTT_FORWARD : B200_NTT_INVERSE, &c, out));
   }
@@ -259,7 +262,7 @@ REGISTER_BIT_REVERSE_BACKEND(B200_DEVICE_TYPE, bit_rev);
 REGISTER_SLICE_BACKEND(B200_DEVICE_TYPE, slice_op);
 REGISTER_MATRIX_TRANSPOSE_BACKEND(B200_DEVICE_TYPE, transpose);
 REGISTER_MATMUL_BACKEND(B200_DEVICE_TYPE, matmul);
-#ifdef B200_HAS_EXT4
+#ifdef B200_HAS_EXT
 REGISTER_VECTOR_ADD_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_vec2<B200_VEC_ADD>);
 REGISTER_VECTOR_SUB_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_vec2<B200_VEC_SUB>);
 REGISTER_VECTOR_MUL_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_vec2<B200_VEC_MUL>);

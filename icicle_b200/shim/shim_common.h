@@ -66,13 +66,16 @@ namespace b200_shim {
 #endif
   }
 
-  // quartic extension of the build's scalar field (EXT_FIELD builds of babybear / koalabear), -1 if we have none
+  // extension field of the build's scalar field (EXT_FIELD builds): the quartic extensions of babybear / koalabear, the
+  // quadratic extension of goldilocks; -1 if we have none
   constexpr int ext_field_id()
   {
 #if FIELD_ID == BABY_BEAR
     return B200_FIELD_BABYBEAR_EXT4;
 #elif FIELD_ID == KOALA_BEAR
     return B200_FIELD_KOALABEAR_EXT4;
+#elif FIELD_ID == GOLDILOCKS
+    return B200_FIELD_GOLDILOCKS_EXT2;
 #else
     return -1;
 #endif
