@@ -12,7 +12,7 @@ import enum
 import numpy as np
 
 from . import capi
-from .capi import IcicleError, MatMulConfigC, MsmConfigC, NttConfigC, VecOpsConfigC, lib, check
+from .capi import IcicleError, HashConfigC, MatMulConfigC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, VecOpsConfigC, lib, check
 
 
 class Field(enum.IntEnum):
@@ -665,6 +665,103 @@ def matmul(field, a, rows_a, cols_a, b, rows_b, cols_b, config=None, output=None
     c = cfg._c()
     check(lib.b200_matmul(int(field), ap, int(rows_a), int(cols_a), bp, int(rows_b), int(cols_b), C.byref(c), op), "matmul")
     return output
+
+
+class HashConfig:
+    """icicle::HashConfig (icicle/include/icicle/hash/hash_config.h:15-24); defaults of default_hash_config()."""
+
+    def __init__(self, **kw):
+        self.stream = None
+        self.batch = 1
+        self.are_inputs_on_device = False
+        self.are_outputs_on_device = False
+        self.is_async = False
+        for k, v in kw.items():
+            if not hasattr(self, k):
+                raise TypeError(f"HashConfig has no field {k}")
+            setattr(self, k, v)
+
+    def _c(self):
+        c = HashConfigC()
+        lib.b200_hash_default_config(C.byref(c))
+        c.stream = _stream_handle(self.stream)
+        c.batch = int(self.batch)
+        for name in ("are_inputs_on_device", "are_outputs_on_device", "is_async"):
+            setattr(c, name, 1 if getattr(self, name) else 0)
+        return c
+
+
+class Poseidon2:
+    """A Poseidon2 hasher of one field (icicle::Poseidon2, icicle/include/icicle/hash/poseidon2.h; the reference's
+    <prefix>_create_poseidon2_hasher).  `constants` is a mapping with the entries of the reference's
+    <field>_poseidon2.h for width t: alpha, upper_full_rounds, partial_rounds, bottom_full_rounds, and the standard-form
+    limb arrays round_constants ((upper + bottom) * t + partial elements), mds_matrix (t * t) and
+    partial_matrix_diagonal (t).  The library holds no constants of its own."""
+
+    def __init__(self, field, t, handle, input_size):
+        self.field, self.t, self._handle, self.input_size = Field(field), int(t), handle, int(input_size)
+
+    @classmethod
+    def create(cls, field, t, constants, domain_tag=None, input_size=0):
+        lim = field_limbs(field)
+        keep = []
+
+        def arr(name):
+            a = np.ascontiguousarray(np.asarray(constants[name], dtype=np.uint32).reshape(-1, lim))
+            keep.append(a)
+            return a.ctypes.data
+
+        c = Poseidon2ConstantsC()
+        c.t, c.alpha = int(t), int(constants["alpha"])
+        c.upper_full_rounds, c.partial_rounds = int(constants["upper_full_rounds"]), int(constants["partial_rounds"])
+        c.bottom_full_rounds = int(constants["bottom_full_rounds"])
+        c.round_constants, c.mds_matrix = arr("round_constants"), arr("mds_matrix")
+        c.partial_matrix_diagonal = arr("partial_matrix_diagonal")
+        tag = None
+        if domain_tag is not None:
+            tag = np.ascontiguousarray(np.asarray(domain_tag, dtype=np.uint32).reshape(lim))
+        h = C.c_void_p()
+        check(lib.b200_poseidon2_create(int(field), C.byref(c), None if tag is None else tag.ctypes.data, int(input_size),
+                                        C.byref(h)), "poseidon2_create")
+        return cls(field, t, h, input_size)
+
+    @property
+    def output_size(self):
+        """bytes of one hash (one field element)"""
+        return 4 * field_limbs(self.field)
+
+    def hash(self, input, size, config=None, output=None):
+        """config.batch hashes of `size` field elements each (input: batch * size elements, contiguous).  Returns output,
+        (batch, limbs), on the device when config.are_outputs_on_device."""
+        if self._handle is None:
+            raise ValueError("Poseidon2 hasher is closed")
+        cfg = copy.copy(config) if config else HashConfig()
+        ip, i_dev, _ki = _ptr(input)
+        cfg.are_inputs_on_device = i_dev
+        if output is None:
+            output = _out_like(self.field, int(cfg.batch), cfg.are_outputs_on_device)
+        op, o_dev, _ko = _out_ptr(output)
+        cfg.are_outputs_on_device = o_dev
+        c = cfg._c()
+        check(lib.b200_poseidon2_hash(self._handle, ip, int(size) * 4 * field_limbs(self.field), C.byref(c), op), "poseidon2_hash")
+        return output
+
+    def close(self):
+        if self._handle is not None:
+            check(lib.b200_poseidon2_destroy(self._handle), "poseidon2_destroy")
+            self._handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def slice(field, a, offset, stride, size_in, size_out, config=None, output=None):

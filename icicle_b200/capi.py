@@ -57,6 +57,21 @@ class MatMulConfigC(C.Structure):
     ]
 
 
+class HashConfigC(C.Structure):
+    _fields_ = [
+        ("stream", C.c_void_p), ("batch", C.c_uint64), ("are_inputs_on_device", C.c_uint8), ("are_outputs_on_device", C.c_uint8),
+        ("is_async", C.c_uint8), ("reserved", C.c_uint8 * 5),
+    ]
+
+
+class Poseidon2ConstantsC(C.Structure):
+    _fields_ = [
+        ("t", C.c_uint), ("alpha", C.c_uint), ("upper_full_rounds", C.c_uint), ("partial_rounds", C.c_uint),
+        ("bottom_full_rounds", C.c_uint), ("round_constants", C.c_void_p), ("mds_matrix", C.c_void_p),
+        ("partial_matrix_diagonal", C.c_void_p),
+    ]
+
+
 # every symbol include/icicle_b200.h declares: name -> (restype, argtypes)
 _vp, _i, _u64, _u32, _sz = C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.c_size_t
 SYMBOLS = {
@@ -110,6 +125,10 @@ SYMBOLS = {
     "b200_matrix_transpose": (_i, [_i, _vp, _u32, _u32, C.POINTER(VecOpsConfigC), _vp]),
     "b200_matmul_default_config": (None, [C.POINTER(MatMulConfigC)]),
     "b200_matmul": (_i, [_i, _vp, _u32, _u32, _vp, _u32, _u32, C.POINTER(MatMulConfigC), _vp]),
+    "b200_hash_default_config": (None, [C.POINTER(HashConfigC)]),
+    "b200_poseidon2_create": (_i, [_i, C.POINTER(Poseidon2ConstantsC), _vp, C.c_uint, C.POINTER(_vp)]),
+    "b200_poseidon2_hash": (_i, [_vp, _vp, _u64, C.POINTER(HashConfigC), _vp]),
+    "b200_poseidon2_destroy": (_i, [_vp]),
     "b200_slice": (_i, [_i, _vp, _u64, _u64, _u64, _u64, C.POINTER(VecOpsConfigC), _vp]),
     "b200_affine_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),
     "b200_projective_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),

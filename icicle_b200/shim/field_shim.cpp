@@ -3,8 +3,10 @@
 //   REGISTER_NTT_BACKEND, REGISTER_NTT_EXT_FIELD_BACKEND (EXT_FIELD builds), REGISTER_NTT_INIT_DOMAIN_BACKEND, REGISTER_NTT_RELEASE_DOMAIN_BACKEND,
 //   REGISTER_NTT_GET_ROU_FROM_DOMAIN_BACKEND, REGISTER_VECTOR_{ADD,ACCUMULATE,SUB,MUL}_BACKEND,
 //   REGISTER_SCALAR_{MUL,ADD,SUB}_VEC_BACKEND, REGISTER_VECTOR_{INV,DIV,SUM,PRODUCT}_BACKEND, REGISTER_CONVERT_MONTGOMERY_BACKEND, REGISTER_BIT_REVERSE_BACKEND,
-//   REGISTER_SLICE_BACKEND, REGISTER_MATRIX_TRANSPOSE_BACKEND, REGISTER_MATMUL_BACKEND.
+//   REGISTER_SLICE_BACKEND, REGISTER_MATRIX_TRANSPOSE_BACKEND, REGISTER_MATMUL_BACKEND,
+//   REGISTER_CREATE_POSEIDON2_BACKEND (POSEIDON2 builds; backend/hash/poseidon2_backend.h:49-65).
 // Each lambda translates the reference config (ntt.h:52-64, vec_ops.h:19-44, mat_ops.h:20-30) to the C structs and forwards.
+#include <vector>
 #include "shim_common.h"
 #include "icicle/vec_ops.h"
 #include "icicle/backend/vec_ops_backend.h"
@@ -279,6 +281,134 @@ REGISTER_CONVERT_MONTGOMERY_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_convert_mont
 REGISTER_MATRIX_TRANSPOSE_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_transpose);
 REGISTER_BIT_REVERSE_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_bit_rev);
 REGISTER_SLICE_EXT_FIELD_BACKEND(B200_DEVICE_TYPE, ext_slice);
+#endif
+#ifdef POSEIDON2
+// Poseidon2: the constants come from the reference header of this build's field, the one its CPU backend uses
+// (icicle/backend/cpu/src/hash/cpu_poseidon2.cpp:4-36) -- i.e. from the installed ICICLE this shim is compiled against.
+// libicicle_b200 holds no constants of its own.
+  #include "icicle/backend/hash/poseidon2_backend.h"
+  #if FIELD_ID == BN254
+    #include "icicle/hash/poseidon2_constants/constants/bn254_poseidon2.h"
+using namespace poseidon2_constants_bn254;
+  #elif FIELD_ID == BLS12_381
+    #include "icicle/hash/poseidon2_constants/constants/bls12_381_poseidon2.h"
+using namespace poseidon2_constants_bls12_381;
+  #elif FIELD_ID == BLS12_377
+    #include "icicle/hash/poseidon2_constants/constants/bls12_377_poseidon2.h"
+using namespace poseidon2_constants_bls12_377;
+  #elif FIELD_ID == BW6_761
+    #include "icicle/hash/poseidon2_constants/constants/bw6_761_poseidon2.h"
+using namespace poseidon2_constants_bw6_761;
+  #elif FIELD_ID == GRUMPKIN
+    #include "icicle/hash/poseidon2_constants/constants/grumpkin_poseidon2.h"
+using namespace poseidon2_constants_grumpkin;
+  #elif FIELD_ID == M31
+    #include "icicle/hash/poseidon2_constants/constants/m31_poseidon2.h"
+using namespace poseidon2_constants_m31;
+  #elif FIELD_ID == BABY_BEAR
+    #include "icicle/hash/poseidon2_constants/constants/babybear_poseidon2.h"
+using namespace poseidon2_constants_babybear;
+  #elif FIELD_ID == STARK_252
+    #include "icicle/hash/poseidon2_constants/constants/stark252_poseidon2.h"
+using namespace poseidon2_constants_stark252;
+  #elif FIELD_ID == KOALA_BEAR
+    #include "icicle/hash/poseidon2_constants/constants/koalabear_poseidon2.h"
+using namespace poseidon2_constants_koalabear;
+  #elif FIELD_ID == GOLDILOCKS
+    #include "icicle/hash/poseidon2_constants/constants/goldilocks_poseidon2.h"
+using namespace poseidon2_constants_goldilocks;
+  #endif
+
+namespace {
+  // Owns one b200 handle; hash() forwards the HashConfig (hash_config.h:15-24) as a b200_hash_config.
+  class B200Poseidon2 : public HashBackend
+  {
+  public:
+    // name, output size and default input chunk size as in the CPU constructor (cpu_poseidon2.cpp:43-51)
+    B200Poseidon2(b200_poseidon2_handle h, unsigned t, bool has_tag, unsigned input_size)
+        : HashBackend("Poseidon2-" B200_DEVICE_TYPE, sizeof(scalar_t), sizeof(scalar_t) * (input_size ? input_size : (has_tag ? t - 1 : t))),
+          m_handle(h)
+    {
+    }
+    ~B200Poseidon2() override { b200_poseidon2_destroy(m_handle); }
+
+    eIcicleError hash(const std::byte* input, uint64_t size, const HashConfig& config, std::byte* output) const override
+    {
+      b200_hash_config c;
+      b200_hash_default_config(&c);
+      c.stream = config.stream;
+      c.batch = config.batch;
+      c.are_inputs_on_device = config.are_inputs_on_device;
+      c.are_outputs_on_device = config.are_outputs_on_device;
+      c.is_async = config.is_async;
+      return to_err(b200_poseidon2_hash(m_handle, input, size, &c, output));
+    }
+
+  private:
+    b200_poseidon2_handle m_handle;
+  };
+
+  std::vector<scalar_t> parse_hex(const std::string* hex, size_t n)
+  {
+    std::vector<scalar_t> v(n);
+    for (size_t i = 0; i < n; i++)
+      v[i] = scalar_t::hex_str2scalar(hex[i]);
+    return v;
+  }
+
+  eIcicleError create_poseidon2(
+    const Device&, unsigned t, const scalar_t* domain_tag, unsigned input_size, std::shared_ptr<HashBackend>& backend)
+  {
+    unsigned alpha, half_full_rounds, partial_rounds;
+    const std::string *rc, *mds, *diag;
+    switch (t) {
+  #define B200_P2_TABLE(T)                                                                                             \
+    case T:                                                                                                            \
+      alpha = alpha_##T;                                                                                               \
+      half_full_rounds = half_full_rounds_##T;                                                                         \
+      partial_rounds = partial_rounds_##T;                                                                             \
+      rc = rounds_constants_##T;                                                                                       \
+      mds = mds_matrix_##T;                                                                                            \
+      diag = partial_matrix_diagonal_##T;                                                                              \
+      break;
+      B200_P2_TABLE(2)
+      B200_P2_TABLE(3)
+      B200_P2_TABLE(4)
+      B200_P2_TABLE(8)
+      B200_P2_TABLE(12)
+      B200_P2_TABLE(16)
+      B200_P2_TABLE(20)
+      B200_P2_TABLE(24)
+  #undef B200_P2_TABLE
+    default:
+      return eIcicleError::INVALID_ARGUMENT;
+    }
+    // the wide fields' tables for t >= 12 are empty with zero round counts: the handle's hash() then refuses, as the
+    // reference's does (cpu_poseidon2.cpp:151-154,188-192)
+    const bool empty = half_full_rounds == 0 && partial_rounds == 0;
+    std::vector<scalar_t> rcv, mdsv, diagv;
+    if (!empty) {
+      rcv = parse_hex(rc, 2 * half_full_rounds * t + partial_rounds);
+      mdsv = parse_hex(mds, (size_t)t * t);
+      diagv = parse_hex(diag, t);
+    }
+    b200_poseidon2_constants c{};
+    c.t = t;
+    c.alpha = alpha;
+    c.upper_full_rounds = c.bottom_full_rounds = half_full_rounds;
+    c.partial_rounds = partial_rounds;
+    c.round_constants = empty ? nullptr : rcv.data();
+    c.mds_matrix = empty ? nullptr : mdsv.data();
+    c.partial_matrix_diagonal = empty ? nullptr : diagv.data();
+    b200_poseidon2_handle h = nullptr;
+    const int err = b200_poseidon2_create(FIELD, &c, domain_tag, input_size, &h);
+    if (err) return to_err(err);
+    backend = std::make_shared<B200Poseidon2>(h, t, domain_tag != nullptr, input_size);
+    return eIcicleError::SUCCESS;
+  }
+} // namespace
+
+REGISTER_CREATE_POSEIDON2_BACKEND(B200_DEVICE_TYPE, create_poseidon2);
 #endif
 #ifdef NTT
 REGISTER_NTT_BACKEND(B200_DEVICE_TYPE, ntt_impl);

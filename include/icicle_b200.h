@@ -275,6 +275,58 @@ typedef struct {
 B200_API void b200_matmul_default_config(b200_matmul_config* cfg);     /* default_mat_mul_config(), mat_ops.h:37 */
 B200_API int b200_matmul(int field, const void* a, uint32_t rows_a, uint32_t cols_a, const void* b, uint32_t rows_b, uint32_t cols_b,
                          const b200_matmul_config* cfg, void* out);
+/* ------------------------------------------------------------------------------------------------------------------
+ * Poseidon2 hash -- replaces the CreatePoseidon2Impl hook (REGISTER_CREATE_POSEIDON2_BACKEND, icicle/include/icicle/backend/
+ * hash/poseidon2_backend.h:49-65; frontend <prefix>_create_poseidon2_hasher, icicle/src/hash/poseidon2_c_api.cpp) and the
+ * HashBackend::hash it returns (backend/hash/hash_backend.h:17-76), i.e. Poseidon2BackendCPU (icicle/backend/cpu/src/hash/
+ * cpu_poseidon2.cpp:38-525).  Fields: BN254_FR, BN254_FQ, BLS12_381_FR, BLS12_377_FR, BLS12_377_FQ, STARK252, BABYBEAR,
+ * KOALABEAR, M31, GOLDILOCKS (the reference's Poseidon2 families; other ids give API_NOT_IMPLEMENTED).
+ * b200_hash_config mirrors icicle::HashConfig (icicle/include/icicle/hash/hash_config.h:15-24); `ext` has no counterpart.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef struct {
+  void* stream;
+  uint64_t batch;              /* number of independent hashes; 0 = nothing to do */
+  uint8_t are_inputs_on_device;
+  uint8_t are_outputs_on_device;
+  uint8_t is_async;
+  uint8_t reserved[5];
+} b200_hash_config;
+
+/* The constants of one Poseidon2 instance, as the reference's hash/poseidon2_constants/constants/<field>_poseidon2.h holds
+ * them (there: rounds_constants_<t>, mds_matrix_<t>, partial_matrix_diagonal_<t>, alpha_<t>, half_full_rounds_<t> for both
+ * the upper and the bottom full rounds, partial_rounds_<t>).  Elements are standard-form limbs of the field. */
+typedef struct {
+  unsigned t;                  /* width: 2, 3, 4, 8, 12, 16, 20 or 24 */
+  unsigned alpha;              /* S-box degree */
+  unsigned upper_full_rounds;
+  unsigned partial_rounds;
+  unsigned bottom_full_rounds;
+  const void* round_constants; /* (upper + bottom) * t + partial elements, in round order (a full round takes t) */
+  const void* mds_matrix;      /* t * t elements, row-major: the external matrix */
+  const void* partial_matrix_diagonal; /* t elements: the internal matrix is J + diag(d) - I, i.e. s_i <- sum(s) + (d_i - 1) s_i */
+} b200_poseidon2_constants;
+
+typedef struct b200_poseidon2* b200_poseidon2_handle;
+
+B200_API void b200_hash_default_config(b200_hash_config* cfg);    /* default_hash_config(), hash_config.h:33: batch = 1 */
+/* Converts the constants once and keeps them on the host (the handle works on any device).  domain_tag: NULL, or one
+ * standard-form element placed in state[0] (the hash then takes t-1 inputs).  input_size: recorded for the caller's
+ * default chunk size only (cpu_poseidon2.cpp:43-51).  INVALID_ARGUMENT when t is not one of the eight widths, the matrix
+ * is not the structured Poseidon2 matrix (t=2: [[2,1],[1,2]]; t=3: 2I+J; t=4: M4 = [[5,7,1,3],[4,6,1,1],[1,3,5,7],[1,1,4,6]];
+ * t>=8: circ(2*M4, M4, ..., M4) in 4x4 blocks), alpha is not the field's S-box degree (BLS12_377_FR 11; STARK252, KOALABEAR
+ * 3; BABYBEAR, GOLDILOCKS 7; the others 5), t > 8 for a field wider than 64 bits, or an element is not canonical.  All-zero
+ * round counts (the reference's empty tables for the wide fields at t >= 12) give a handle whose hash returns
+ * INVALID_ARGUMENT, as the reference's does (cpu_poseidon2.cpp:188-192). */
+B200_API int b200_poseidon2_create(int field, const b200_poseidon2_constants* constants, const void* domain_tag,
+                                   unsigned input_size, b200_poseidon2_handle* handle);
+/* cfg->batch hashes of size_bytes each (input: batch * size_bytes contiguous bytes), one element out per hash.  A row of
+ * t elements (t-1 with a domain tag) is one permutation; any other length runs the reference's sponge with [1,0,..]
+ * padding (cpu_poseidon2.cpp:184-262,453-518).  INVALID_ARGUMENT when size_bytes is 0 or not a whole number of elements
+ * (the reference reads past the input there). */
+B200_API int b200_poseidon2_hash(b200_poseidon2_handle handle, const void* input, uint64_t size_bytes, const b200_hash_config* cfg,
+                                 void* output);
+B200_API int b200_poseidon2_destroy(b200_poseidon2_handle handle);
+
 /* slice (cpu_vec_ops.cpp:577-596): out[i] = in[offset + i*stride] */
 B200_API int b200_slice(int field, const void* in, uint64_t offset, uint64_t stride, uint64_t size_in, uint64_t size_out,
                const b200_vec_ops_config* cfg, void* out);
