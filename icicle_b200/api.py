@@ -12,7 +12,7 @@ import enum
 import numpy as np
 
 from . import capi
-from .capi import IcicleError, HashConfigC, MatMulConfigC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, VecOpsConfigC, lib, check
+from .capi import IcicleError, HashConfigC, MatMulConfigC, MerkleConfigC, MerkleLayerC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, VecOpsConfigC, lib, check
 
 
 class Field(enum.IntEnum):
@@ -749,6 +749,142 @@ class Poseidon2:
     def close(self):
         if self._handle is not None:
             check(lib.b200_poseidon2_destroy(self._handle), "poseidon2_destroy")
+            self._handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class PaddingPolicy(enum.IntEnum):  # icicle/include/icicle/merkle/merkle_tree_config.h:11-16
+    NONE = 0
+    ZERO_PADDING = 1
+    LAST_VALUE = 2
+
+
+class MerkleTreeConfig:
+    """icicle::MerkleTreeConfig (icicle/include/icicle/merkle/merkle_tree_config.h:18-37); defaults of
+    default_merkle_tree_config(): leaves on the host, tree on the device, synchronous, no padding."""
+
+    def __init__(self, **kw):
+        self.stream = None
+        self.is_leaves_on_device = False
+        self.is_tree_on_device = True
+        self.is_async = False
+        self.padding_policy = PaddingPolicy.NONE
+        for k, v in kw.items():
+            if not hasattr(self, k):
+                raise TypeError(f"MerkleTreeConfig has no field {k}")
+            setattr(self, k, v)
+
+    def _c(self):
+        c = MerkleConfigC()
+        lib.b200_merkle_default_config(C.byref(c))
+        c.stream = _stream_handle(self.stream)
+        for name in ("is_leaves_on_device", "is_tree_on_device", "is_async"):
+            setattr(c, name, 1 if getattr(self, name) else 0)
+        c.padding_policy = int(self.padding_policy)
+        return c
+
+
+def _nbytes(x):
+    return x.numel() * x.element_size() if _is_torch(x) else x.nbytes
+
+
+def _byte_out(nbytes, on_device):
+    if on_device:
+        import torch
+        return torch.empty(int(nbytes), dtype=torch.uint8, device="cuda")
+    return np.empty(int(nbytes), dtype=np.uint8)
+
+
+class MerkleTree:
+    """A Merkle tree whose layers are Poseidon2 hashers (icicle::MerkleTree, icicle/include/icicle/merkle/merkle_tree.h;
+    the reference's icicle_merkle_tree_create).  layers[0] hashes the leaves, the last layer gives the root; every hash runs
+    on the GPU.  Byte-oriented like the reference: leaf_element_size and every size are in bytes, roots and proofs are uint8
+    arrays (numpy on the host, torch on the device).  The hashers must stay open while the tree is used."""
+
+    def __init__(self, handle, layers, leaf_element_size, output_store_min_layer):
+        self._handle, self.layers = handle, list(layers)
+        self.leaf_element_size, self.output_store_min_layer = int(leaf_element_size), int(output_store_min_layer)
+
+    @classmethod
+    def create(cls, layers, leaf_element_size, output_store_min_layer=0):
+        arr = (MerkleLayerC * len(layers))()
+        for i, h in enumerate(layers):
+            if not isinstance(h, Poseidon2) or h._handle is None:
+                raise ValueError("MerkleTree layers must be open Poseidon2 hashers")
+            check(lib.b200_poseidon2_merkle_layer(h._handle, C.byref(arr[i])), "poseidon2_merkle_layer")
+        t = C.c_void_p()
+        check(lib.b200_merkle_tree_create(arr, len(layers), int(leaf_element_size), int(output_store_min_layer), C.byref(t)),
+              "merkle_tree_create")
+        return cls(t, layers, leaf_element_size, output_store_min_layer)
+
+    def _h(self):
+        if self._handle is None:
+            raise ValueError("Merkle tree is closed")
+        return self._handle
+
+    def build(self, leaves, leaves_size=None, config=None):
+        """Builds the tree over the first leaves_size bytes of `leaves` (default: all of it), host or device."""
+        cfg = copy.copy(config) if config else MerkleTreeConfig()
+        lp, l_dev, _kl = _ptr(leaves)
+        cfg.is_leaves_on_device = l_dev
+        n = _nbytes(_kl) if leaves_size is None else leaves_size
+        c = cfg._c()
+        check(lib.b200_merkle_tree_build(self._h(), lp, int(n), C.byref(c)), "merkle_tree_build")
+
+    @property
+    def root_size(self):
+        n = C.c_uint64()
+        check(lib.b200_merkle_tree_root_size(self._h(), C.byref(n)), "merkle_tree_root_size")
+        return n.value
+
+    def root(self, on_device=False):
+        out = _byte_out(self.root_size, on_device)
+        check(lib.b200_merkle_tree_get_root(self._h(), _ptr(out)[0], 1 if on_device else 0), "merkle_tree_get_root")
+        return out
+
+    def proof_sizes(self, pruned=False):
+        """(leaf bytes, path bytes) of one proof"""
+        a, b = C.c_uint64(), C.c_uint64()
+        check(lib.b200_merkle_tree_proof_sizes(self._h(), 1 if pruned else 0, C.byref(a), C.byref(b)), "merkle_tree_proof_sizes")
+        return a.value, b.value
+
+    def proofs(self, leaves, leaf_indices, pruned=False, config=None, leaves_size=None, on_device=False):
+        """Proofs of every leaf index at once: (leaf, path) with leaf (n, leaf bytes) and path (n, path bytes), uint8.
+        `leaves` and the config's padding policy are those of the build."""
+        cfg = copy.copy(config) if config else MerkleTreeConfig()
+        lp, l_dev, _kl = _ptr(leaves)
+        cfg.is_leaves_on_device = l_dev
+        if leaves_size is None:
+            leaves_size = _nbytes(_kl)
+        idx = np.ascontiguousarray(np.asarray(leaf_indices, dtype=np.uint64).reshape(-1))
+        n = idx.size
+        lb, pb = self.proof_sizes(pruned)
+        leaf, path = _byte_out(n * lb, on_device), _byte_out(max(1, n * pb), on_device)
+        c = cfg._c()
+        check(lib.b200_merkle_tree_get_proofs(self._h(), lp, int(leaves_size), idx.ctypes.data_as(C.POINTER(C.c_uint64)), n,
+                                              1 if pruned else 0, C.byref(c), _ptr(leaf)[0], _ptr(path)[0]),
+              "merkle_tree_get_proofs")
+        return leaf.reshape(n, lb), path[:n * pb].reshape(n, pb)
+
+    def proof(self, leaves, leaf_idx, pruned=False, config=None, leaves_size=None):
+        """One proof: (leaf bytes, path bytes) as 1-D uint8 numpy arrays."""
+        leaf, path = self.proofs(leaves, [leaf_idx], pruned, config, leaves_size)
+        return leaf[0], path[0]
+
+    def close(self):
+        if self._handle is not None:
+            check(lib.b200_merkle_tree_destroy(self._handle), "merkle_tree_destroy")
             self._handle = None
 
     def __enter__(self):

@@ -72,6 +72,17 @@ class Poseidon2ConstantsC(C.Structure):
     ]
 
 
+class MerkleLayerC(C.Structure):
+    _fields_ = [("input_chunk_bytes", C.c_uint64), ("output_bytes", C.c_uint64), ("hash", C.c_void_p), ("ctx", C.c_void_p)]
+
+
+class MerkleConfigC(C.Structure):
+    _fields_ = [
+        ("stream", C.c_void_p), ("is_leaves_on_device", C.c_uint8), ("is_tree_on_device", C.c_uint8), ("is_async", C.c_uint8),
+        ("reserved", C.c_uint8), ("padding_policy", C.c_int),
+    ]
+
+
 # every symbol include/icicle_b200.h declares: name -> (restype, argtypes)
 _vp, _i, _u64, _u32, _sz = C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.c_size_t
 SYMBOLS = {
@@ -129,6 +140,15 @@ SYMBOLS = {
     "b200_poseidon2_create": (_i, [_i, C.POINTER(Poseidon2ConstantsC), _vp, C.c_uint, C.POINTER(_vp)]),
     "b200_poseidon2_hash": (_i, [_vp, _vp, _u64, C.POINTER(HashConfigC), _vp]),
     "b200_poseidon2_destroy": (_i, [_vp]),
+    "b200_merkle_default_config": (None, [C.POINTER(MerkleConfigC)]),
+    "b200_poseidon2_merkle_layer": (_i, [_vp, C.POINTER(MerkleLayerC)]),
+    "b200_merkle_tree_create": (_i, [C.POINTER(MerkleLayerC), C.c_uint, _u64, _u64, C.POINTER(_vp)]),
+    "b200_merkle_tree_build": (_i, [_vp, _vp, _u64, C.POINTER(MerkleConfigC)]),
+    "b200_merkle_tree_get_root": (_i, [_vp, _vp, _i]),
+    "b200_merkle_tree_root_size": (_i, [_vp, C.POINTER(_u64)]),
+    "b200_merkle_tree_proof_sizes": (_i, [_vp, _i, C.POINTER(_u64), C.POINTER(_u64)]),
+    "b200_merkle_tree_get_proofs": (_i, [_vp, _vp, _u64, C.POINTER(_u64), _u64, _i, C.POINTER(MerkleConfigC), _vp, _vp]),
+    "b200_merkle_tree_destroy": (_i, [_vp]),
     "b200_slice": (_i, [_i, _vp, _u64, _u64, _u64, _u64, C.POINTER(VecOpsConfigC), _vp]),
     "b200_affine_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),
     "b200_projective_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),

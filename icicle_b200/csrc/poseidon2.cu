@@ -408,4 +408,25 @@ int b200_poseidon2_destroy(b200_poseidon2_handle handle)
   return B200_SUCCESS;
 }
 
+// A Merkle layer hashes device chunks into device outputs on the tree's stream, without synchronising.
+static int p2_merkle_hash(void* ctx, const void* in, uint64_t chunk_bytes, uint64_t batch, void* out, void* stream)
+{
+  b200_hash_config c;
+  b200_hash_default_config(&c);
+  c.stream = stream;
+  c.batch = batch;
+  c.are_inputs_on_device = c.are_outputs_on_device = c.is_async = 1;
+  return b200_poseidon2_hash((b200_poseidon2_handle)ctx, in, chunk_bytes, &c, out);
+}
+
+int b200_poseidon2_merkle_layer(b200_poseidon2_handle handle, b200_merkle_layer* out)
+{
+  if (!handle || !out) return B200_INVALID_POINTER;
+  const uint64_t elem = (uint64_t)b200_field_bytes(handle->field);
+  // default input chunk as the shim's B200Poseidon2 (and cpu_poseidon2.cpp:43-51) sets it
+  const uint64_t inputs = handle->input_size ? handle->input_size : (handle->has_tag ? handle->t - 1 : handle->t);
+  *out = b200_merkle_layer{inputs * elem, elem, p2_merkle_hash, handle};
+  return B200_SUCCESS;
+}
+
 } // extern "C"

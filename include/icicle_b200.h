@@ -327,6 +327,70 @@ B200_API int b200_poseidon2_hash(b200_poseidon2_handle handle, const void* input
                                  void* output);
 B200_API int b200_poseidon2_destroy(b200_poseidon2_handle handle);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Merkle tree -- replaces the MerkleTreeFactoryImpl hook (REGISTER_MERKLE_TREE_FACTORY_BACKEND, icicle/include/icicle/
+ * backend/merkle/merkle_tree_backend.h; frontend icicle/src/hash/merkle_tree.cpp, merkle_c_api.cpp) and the
+ * MerkleTreeBackend it returns, i.e. CPUMerkleTreeBackend (icicle/backend/cpu/src/hash/cpu_merkle_tree.cpp), byte for byte:
+ * roots, stored layers, proof leaves and proof paths, pruned and full.
+ * The library does not know which hash a layer runs: each layer is a descriptor with a callback that hashes `batch`
+ * contiguous chunks of `chunk_bytes` bytes from device memory into `batch` outputs of `output_bytes` in device memory,
+ * enqueued on `stream` without synchronising.  b200_poseidon2_merkle_layer() gives that descriptor for a Poseidon2 handle.
+ * Shape (cpu_merkle_tree.cpp:27-50): n_top = 1 hash, n_{l-1} = n_l * chunk_l / output_{l-1}; the tree takes up to
+ * n_0 * chunk_0 leaf bytes.  Layer l runs r_l = min(n_l, ceil(size_l / chunk_l) + 1) hashes (size_0 = leaves_size,
+ * size_{l+1} = ceil(size_l / chunk_l) * output_l); its stored array holds r_{l+1} * chunk_{l+1} bytes (the root: output
+ * bytes), the tail past its r_l hashes filled with copies of the last one (cpu_merkle_tree.cpp:359-415, 521-533).  Layer-0
+ * bytes past leaves_size are 0 (ZeroPadding) or repeat the last leaf element (LastValue).  Only layers >=
+ * output_store_min_layer are kept; proofs rebuild the sub-trees below from the leaves.
+ * ---------------------------------------------------------------------------------------------------------------- */
+typedef int (*b200_merkle_hash_fn)(void* ctx, const void* in_dev, uint64_t chunk_bytes, uint64_t batch, void* out_dev,
+                                   void* stream);
+typedef struct {
+  uint64_t input_chunk_bytes;  /* Hash::default_input_chunk_size() */
+  uint64_t output_bytes;       /* Hash::output_size() */
+  b200_merkle_hash_fn hash;
+  void* ctx;                   /* passed to hash(); must outlive the tree */
+} b200_merkle_layer;
+
+enum { B200_PADDING_NONE = 0, B200_PADDING_ZERO = 1, B200_PADDING_LAST_VALUE = 2 }; /* PaddingPolicy, merkle_tree_config.h:11-16 */
+/* mirror of icicle::MerkleTreeConfig (icicle/include/icicle/merkle/merkle_tree_config.h:18-37); `ext` has no counterpart */
+typedef struct {
+  void* stream;
+  uint8_t is_leaves_on_device;
+  uint8_t is_tree_on_device;   /* false: the stored layers are copied to host after the build, their device memory freed */
+  uint8_t is_async;
+  uint8_t reserved;
+  int padding_policy;          /* B200_PADDING_* */
+} b200_merkle_config;
+
+typedef struct b200_merkle_tree* b200_merkle_tree_handle;
+
+B200_API void b200_merkle_default_config(b200_merkle_config* cfg); /* default_merkle_tree_config(): tree on device, no padding */
+/* the layer descriptor of one Poseidon2 handle: chunk = input_size elements (t, or t-1 with a domain tag, when input_size
+ * is 0), output = one element; the handle must outlive every tree made with it */
+B200_API int b200_poseidon2_merkle_layer(b200_poseidon2_handle h, b200_merkle_layer* out);
+/* INVALID_ARGUMENT unless n_layers >= 1, output_store_min_layer < n_layers, chunk_0 % leaf_element_size == 0 and
+ * chunk_{l+1} % output_l == 0 (the reference asserts these, merkle_tree_backend.h and cpu_merkle_tree.cpp:29-34) */
+B200_API int b200_merkle_tree_create(const b200_merkle_layer* layers, unsigned n_layers, uint64_t leaf_element_size,
+                                     uint64_t output_store_min_layer, b200_merkle_tree_handle* tree);
+/* INVALID_ARGUMENT for a second build, leaves_size 0 or above n_0 * chunk_0, below it with B200_PADDING_NONE, or
+ * LastValue with leaves_size % leaf_element_size != 0 (cpu_merkle_tree.cpp:56-59,359-376,440-444) */
+B200_API int b200_merkle_tree_build(b200_merkle_tree_handle tree, const void* leaves, uint64_t leaves_size,
+                                    const b200_merkle_config* cfg);
+/* copies the root (output bytes of the top layer) to `out`; a host `out` waits for the build's stream */
+B200_API int b200_merkle_tree_get_root(b200_merkle_tree_handle tree, void* out, int out_on_device);
+B200_API int b200_merkle_tree_root_size(b200_merkle_tree_handle tree, uint64_t* bytes);
+/* bytes of one proof's leaf (chunk_0) and path (sum over l >= 1 of chunk_l, minus output_{l-1} when pruned) */
+B200_API int b200_merkle_tree_proof_sizes(b200_merkle_tree_handle tree, int pruned, uint64_t* leaf_bytes, uint64_t* path_bytes);
+/* n proofs at once (MerkleTreeBackend::get_merkle_proof is n = 1; cpu_merkle_tree.cpp:143-211,545-573): proof i's leaf
+ * (the padded chunk_0 holding leaf_idx[i]) at leaf_out + i * leaf_bytes, its path at path_out + i * path_bytes.  leaf_idx is
+ * a host array; leaf_out / path_out are host or device memory.  `leaves` is what the tree was built from (host or device,
+ * cfg->is_leaves_on_device); cfg->padding_policy gives the padding.  INVALID_ARGUMENT before the build or for an index at or
+ * past leaves_size / leaf_element_size (the reference only logs that and reads past the leaves). */
+B200_API int b200_merkle_tree_get_proofs(b200_merkle_tree_handle tree, const void* leaves, uint64_t leaves_size,
+                                         const uint64_t* leaf_idx, uint64_t n, int pruned, const b200_merkle_config* cfg,
+                                         void* leaf_out, void* path_out);
+B200_API int b200_merkle_tree_destroy(b200_merkle_tree_handle tree);
+
 /* slice (cpu_vec_ops.cpp:577-596): out[i] = in[offset + i*stride] */
 B200_API int b200_slice(int field, const void* in, uint64_t offset, uint64_t stride, uint64_t size_in, uint64_t size_out,
                const b200_vec_ops_config* cfg, void* out);
