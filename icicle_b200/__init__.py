@@ -5,7 +5,7 @@ C++ registration shims that plug the C ABI into ICICLE's REGISTER_*_BACKEND hook
 reference frontend used by tests/ and bench.py.  Importing it requires the built native library (no fallback).
 """
 from .api import *  # noqa: F401,F403
-from .api import Field, Curve, NTTDir, Ordering, MSMConfig, NTTConfig, VecOpsConfig, MatMulConfig, HashConfig, Poseidon2, MerkleTreeConfig, MerkleTree, PaddingPolicy, IcicleError  # noqa: F401
+from .api import Field, Curve, NTTDir, Ordering, MSMConfig, NTTConfig, VecOpsConfig, MatMulConfig, HashConfig, Poseidon2, MerkleTreeConfig, MerkleTree, PaddingPolicy, HashKind, Hasher, PowConfig, proof_of_work, proof_of_work_verify, IcicleError  # noqa: F401
 from . import utils  # noqa: F401
 
 __version__ = "0.1.0"

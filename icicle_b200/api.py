@@ -12,7 +12,7 @@ import enum
 import numpy as np
 
 from . import capi
-from .capi import IcicleError, HashConfigC, MatMulConfigC, MerkleConfigC, MerkleLayerC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, VecOpsConfigC, lib, check
+from .capi import IcicleError, HashConfigC, MatMulConfigC, MerkleConfigC, MerkleLayerC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, PowConfigC, VecOpsConfigC, lib, check
 
 
 class Field(enum.IntEnum):
@@ -764,6 +764,154 @@ class Poseidon2:
             pass
 
 
+class HashKind(enum.IntEnum):  # b200_hash_kind (include/icicle_b200.h)
+    KECCAK_256 = 0
+    KECCAK_512 = 1
+    SHA3_256 = 2
+    SHA3_512 = 3
+    BLAKE2S = 4
+    BLAKE3 = 5
+
+
+def _byte_buffer(x):
+    """(pointer, on_device, bytes, keepalive) of an input byte buffer: bytes, a numpy array or a torch tensor"""
+    if isinstance(x, (bytes, bytearray)):
+        x = np.frombuffer(bytes(x), dtype=np.uint8)
+    p, dev, keep = _ptr(x)
+    return p, dev, _nbytes(keep), keep
+
+
+class Hasher:
+    """A general-purpose hash (icicle::Keccak256 / Keccak512 / Sha3_256 / Sha3_512 / Blake2s / Blake3,
+    icicle/include/icicle/hash/keccak.h, blake2s.h, blake3.h).  Byte-oriented like MerkleTree: rows and digests are bytes,
+    uint8 numpy arrays on the host and torch tensors on the device.  input_chunk_size is the default row size."""
+
+    def __init__(self, kind, handle, input_chunk_size):
+        self.kind, self._handle, self.input_chunk_size = HashKind(kind), handle, int(input_chunk_size)
+
+    @classmethod
+    def create(cls, kind, input_chunk_size=0):
+        h = C.c_void_p()
+        check(lib.b200_hasher_create(int(kind), int(input_chunk_size), C.byref(h)), "hasher_create")
+        return cls(kind, h, input_chunk_size)
+
+    def _h(self):
+        if self._handle is None:
+            raise ValueError("hasher is closed")
+        return self._handle
+
+    @property
+    def output_size(self):
+        """bytes of one digest"""
+        n = C.c_uint64()
+        check(lib.b200_hasher_output_size(self._h(), C.byref(n)), "hasher_output_size")
+        return n.value
+
+    def hash(self, input, size_bytes=0, config=None, output=None):
+        """config.batch digests of rows of size_bytes each (0: the default chunk), read contiguously from `input` (bytes,
+        numpy or a torch tensor, at any byte offset).  Returns the digests as (batch, output_size) uint8: `output` if given,
+        else a new numpy array, or a torch tensor when config.are_outputs_on_device."""
+        cfg = copy.copy(config) if config else HashConfig()
+        size = int(size_bytes) or self.input_chunk_size
+        ip, i_dev, i_bytes, _ki = _byte_buffer(input)
+        if size and i_bytes < size * int(cfg.batch):
+            raise ValueError(f"input holds {i_bytes} bytes, fewer than batch * size = {int(cfg.batch) * size}")
+        cfg.are_inputs_on_device = i_dev
+        n_out = int(cfg.batch) * self.output_size
+        made = output is None
+        if made:
+            output = _byte_out(n_out, cfg.are_outputs_on_device)
+        elif not _is_torch(output) and (not isinstance(output, np.ndarray) or not output.flags.c_contiguous
+                                        or not output.flags.writeable):
+            raise ValueError("output buffers must be writeable C-contiguous numpy arrays or torch tensors")
+        if _nbytes(output) < n_out:
+            raise ValueError(f"output holds {_nbytes(output)} bytes, fewer than {n_out}")
+        op, o_dev, _ko = _ptr(output)
+        cfg.are_outputs_on_device = o_dev
+        c = cfg._c()
+        check(lib.b200_hasher_hash(self._h(), ip, int(size_bytes), C.byref(c), op), "hasher_hash")
+        return output.reshape(int(cfg.batch), self.output_size) if made else output
+
+    def close(self):
+        if self._handle is not None:
+            check(lib.b200_hasher_destroy(self._handle), "hasher_destroy")
+            self._handle = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _layer_of(h, out):
+    """fills the b200_merkle_layer `out` for an open Poseidon2 or Hasher"""
+    if isinstance(h, Hasher):
+        check(lib.b200_hasher_merkle_layer(h._h(), C.byref(out)), "hasher_merkle_layer")
+    elif isinstance(h, Poseidon2) and h._handle is not None:
+        check(lib.b200_poseidon2_merkle_layer(h._handle, C.byref(out)), "poseidon2_merkle_layer")
+    else:
+        raise ValueError("expected an open Hasher or Poseidon2")
+    return out
+
+
+class PowConfig:
+    """icicle::PowConfig (icicle/include/icicle/hash/pow.h:16-25); defaults of default_pow_config().  is_async is accepted
+    and has no effect: proof_of_work and proof_of_work_verify always return with their results."""
+
+    def __init__(self, **kw):
+        self.stream = None
+        self.is_challenge_on_device = False
+        self.padding_size = 24
+        self.is_async = False
+        for k, v in kw.items():
+            if not hasattr(self, k):
+                raise TypeError(f"PowConfig has no field {k}")
+            setattr(self, k, v)
+
+    def _c(self):
+        c = PowConfigC()
+        lib.b200_pow_default_config(C.byref(c))
+        c.stream = _stream_handle(self.stream)
+        c.is_challenge_on_device = 1 if self.is_challenge_on_device else 0
+        c.is_async = 1 if self.is_async else 0
+        c.padding_size = int(self.padding_size)
+        return c
+
+
+def proof_of_work(hasher, challenge, bits, config=None):
+    """The smallest nonce whose row challenge || nonce (LE u64) || padding zeros hashes, with `hasher` (a Hasher or a
+    Poseidon2), to a digest whose first 8 bytes (LE u64) are below 2^(64 - bits).  Returns (found, nonce, mined_hash)."""
+    cfg = copy.copy(config) if config else PowConfig()
+    cp, c_dev, c_bytes, _kc = _byte_buffer(challenge)
+    cfg.is_challenge_on_device = c_dev
+    layer = _layer_of(hasher, MerkleLayerC())
+    found, nonce, mined = C.c_int(), C.c_uint64(), C.c_uint64()
+    c = cfg._c()
+    check(lib.b200_pow_solve(C.byref(layer), cp, c_bytes, int(bits), C.byref(c), C.byref(found), C.byref(nonce),
+                             C.byref(mined)), "pow_solve")
+    return bool(found.value), nonce.value, mined.value
+
+
+def proof_of_work_verify(hasher, challenge, bits, nonce, config=None):
+    """(is_correct, mined_hash) of one nonce, as proof_of_work defines them."""
+    cfg = copy.copy(config) if config else PowConfig()
+    cp, c_dev, c_bytes, _kc = _byte_buffer(challenge)
+    cfg.is_challenge_on_device = c_dev
+    layer = _layer_of(hasher, MerkleLayerC())
+    ok, mined = C.c_int(), C.c_uint64()
+    c = cfg._c()
+    check(lib.b200_pow_verify(C.byref(layer), cp, c_bytes, int(bits), C.byref(c), int(nonce), C.byref(ok), C.byref(mined)),
+          "pow_verify")
+    return bool(ok.value), mined.value
+
+
 class PaddingPolicy(enum.IntEnum):  # icicle/include/icicle/merkle/merkle_tree_config.h:11-16
     NONE = 0
     ZERO_PADDING = 1
@@ -807,7 +955,7 @@ def _byte_out(nbytes, on_device):
 
 
 class MerkleTree:
-    """A Merkle tree whose layers are Poseidon2 hashers (icicle::MerkleTree, icicle/include/icicle/merkle/merkle_tree.h;
+    """A Merkle tree whose layers are Poseidon2 or Hasher hashes, mixed freely (icicle::MerkleTree, icicle/include/icicle/merkle/merkle_tree.h;
     the reference's icicle_merkle_tree_create).  layers[0] hashes the leaves, the last layer gives the root; every hash runs
     on the GPU.  Byte-oriented like the reference: leaf_element_size and every size are in bytes, roots and proofs are uint8
     arrays (numpy on the host, torch on the device).  The hashers must stay open while the tree is used."""
@@ -820,9 +968,9 @@ class MerkleTree:
     def create(cls, layers, leaf_element_size, output_store_min_layer=0):
         arr = (MerkleLayerC * len(layers))()
         for i, h in enumerate(layers):
-            if not isinstance(h, Poseidon2) or h._handle is None:
-                raise ValueError("MerkleTree layers must be open Poseidon2 hashers")
-            check(lib.b200_poseidon2_merkle_layer(h._handle, C.byref(arr[i])), "poseidon2_merkle_layer")
+            if not isinstance(h, (Poseidon2, Hasher)) or h._handle is None:
+                raise ValueError("MerkleTree layers must be open Poseidon2 or Hasher hashers")
+            _layer_of(h, arr[i])
         t = C.c_void_p()
         check(lib.b200_merkle_tree_create(arr, len(layers), int(leaf_element_size), int(output_store_min_layer), C.byref(t)),
               "merkle_tree_create")

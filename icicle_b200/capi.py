@@ -83,6 +83,13 @@ class MerkleConfigC(C.Structure):
     ]
 
 
+class PowConfigC(C.Structure):
+    _fields_ = [
+        ("stream", C.c_void_p), ("is_challenge_on_device", C.c_uint8), ("is_async", C.c_uint8), ("reserved", C.c_uint8 * 2),
+        ("padding_size", C.c_uint32),
+    ]
+
+
 # every symbol include/icicle_b200.h declares: name -> (restype, argtypes)
 _vp, _i, _u64, _u32, _sz = C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.c_size_t
 SYMBOLS = {
@@ -149,6 +156,16 @@ SYMBOLS = {
     "b200_merkle_tree_proof_sizes": (_i, [_vp, _i, C.POINTER(_u64), C.POINTER(_u64)]),
     "b200_merkle_tree_get_proofs": (_i, [_vp, _vp, _u64, C.POINTER(_u64), _u64, _i, C.POINTER(MerkleConfigC), _vp, _vp]),
     "b200_merkle_tree_destroy": (_i, [_vp]),
+    "b200_hasher_create": (_i, [_i, _u64, C.POINTER(_vp)]),
+    "b200_hasher_hash": (_i, [_vp, _vp, _u64, C.POINTER(HashConfigC), _vp]),
+    "b200_hasher_output_size": (_i, [_vp, C.POINTER(_u64)]),
+    "b200_hasher_destroy": (_i, [_vp]),
+    "b200_hasher_merkle_layer": (_i, [_vp, C.POINTER(MerkleLayerC)]),
+    "b200_pow_default_config": (None, [C.POINTER(PowConfigC)]),
+    "b200_pow_solve": (_i, [C.POINTER(MerkleLayerC), _vp, _u32, C.c_uint8, C.POINTER(PowConfigC), C.POINTER(_i),
+                            C.POINTER(_u64), C.POINTER(_u64)]),
+    "b200_pow_verify": (_i, [C.POINTER(MerkleLayerC), _vp, _u32, C.c_uint8, C.POINTER(PowConfigC), _u64, C.POINTER(_i),
+                             C.POINTER(_u64)]),
     "b200_slice": (_i, [_i, _vp, _u64, _u64, _u64, _u64, C.POINTER(VecOpsConfigC), _vp]),
     "b200_affine_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),
     "b200_projective_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),

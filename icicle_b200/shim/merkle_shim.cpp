@@ -5,7 +5,7 @@
 //
 // The tree does not know which hash a layer runs.  Each layer's icicle::Hash becomes a b200_merkle_layer whose callback
 // calls Hash::hash on device memory, asynchronously, on the build stream.  Only hashes made by this backend are accepted
-// (their name ends in "-" B200_DEVICE_TYPE, as the field shim's B200Poseidon2 sets it): a CPU hash would be handed device
+// (their name ends in "-" B200_DEVICE_TYPE, as the field shim's B200Poseidon2 and hash_shim.cpp's hashes set it): a CPU hash would be handed device
 // pointers.  verify() is frontend code (merkle_tree.h) and runs unchanged on these hashes.
 #include <memory>
 #include <string>
@@ -17,16 +17,6 @@ using namespace icicle;
 using namespace b200_shim;
 
 namespace {
-
-  int hash_on_device(void* ctx, const void* in, uint64_t chunk_bytes, uint64_t batch, void* out, void* stream)
-  {
-    HashConfig c;
-    c.stream = stream;
-    c.batch = batch;
-    c.are_inputs_on_device = c.are_outputs_on_device = c.is_async = true;
-    return (int)static_cast<const Hash*>(ctx)->hash(
-      static_cast<const std::byte*>(in), chunk_bytes, c, static_cast<std::byte*>(out));
-  }
 
   b200_merkle_config to_c(const MerkleTreeConfig& c)
   {
@@ -59,7 +49,7 @@ namespace {
       std::vector<b200_merkle_layer> layers(m_layer_hashes.size());
       for (size_t l = 0; l < layers.size(); l++) {
         const Hash& h = m_layer_hashes[l];
-        layers[l] = b200_merkle_layer{h.default_input_chunk_size(), h.output_size(), hash_on_device, const_cast<Hash*>(&h)};
+        layers[l] = b200_merkle_layer{h.default_input_chunk_size(), h.output_size(), hash_on_device<Hash, HashConfig>, const_cast<Hash*>(&h)};
       }
       const int err =
         b200_merkle_tree_create(layers.data(), (unsigned)layers.size(), m_leaf_element_size, m_output_store_min_layer, &m_tree);
@@ -119,11 +109,6 @@ namespace {
     mutable void* m_root_dev = nullptr;
   };
 
-  bool ends_with(const std::string& s, const std::string& suffix)
-  {
-    return s.size() >= suffix.size() && s.compare(s.size() - suffix.size(), suffix.size(), suffix) == 0;
-  }
-
   eIcicleError create_merkle_tree(
     const Device&,
     const std::vector<Hash>& layer_hashes,
@@ -135,7 +120,7 @@ namespace {
         layer_hashes[0].default_input_chunk_size() % leaf_element_size)
       return eIcicleError::INVALID_ARGUMENT; // what MerkleTreeBackend's constructor asserts
     for (const Hash& h : layer_hashes)
-      if (!ends_with(h.name(), "-" B200_DEVICE_TYPE)) return eIcicleError::INVALID_ARGUMENT; // no fallback to a host hash
+      if (!is_device_hash(h)) return eIcicleError::INVALID_ARGUMENT; // no fallback to a host hash
     auto tree = std::make_shared<B200MerkleTree>(layer_hashes, leaf_element_size, output_store_min_layer);
     const int err = tree->init();
     if (err) return to_err(err);

@@ -21,6 +21,31 @@ namespace b200_shim {
 
   inline icicle::eIcicleError to_err(int code) { return static_cast<icicle::eIcicleError>(code); }
 
+  // b200_merkle_layer callback over an icicle::Hash made by this backend: hashes `batch` device rows into device outputs on
+  // `stream`, without synchronising.  The Merkle-tree and PoW registrations hand the library their Hash objects this way:
+  // hash_on_device<Hash, HashConfig>.  A template, so that only the shims that use it include the hash headers (their
+  // CpuBackendConfig clashes with the MSM config header's in the curve shim).
+  template <class Hash, class HashConfig>
+  int hash_on_device(void* ctx, const void* in, uint64_t chunk_bytes, uint64_t batch, void* out, void* stream)
+  {
+    HashConfig c;
+    c.stream = stream;
+    c.batch = batch;
+    c.are_inputs_on_device = c.are_outputs_on_device = c.is_async = true;
+    return (int)static_cast<const Hash*>(ctx)->hash(
+      static_cast<const std::byte*>(in), chunk_bytes, c, static_cast<std::byte*>(out));
+  }
+
+  // the hashes this backend makes name themselves "<hash>-" B200_DEVICE_TYPE (a host hash would be handed device pointers)
+  template <class Hash>
+  bool is_device_hash(const Hash& h)
+  {
+    const auto& s = h.name();
+    const char* suffix = "-" B200_DEVICE_TYPE;
+    const size_t n = std::strlen(suffix);
+    return s.size() >= n && s.compare(s.size() - n, n, suffix) == 0;
+  }
+
   inline int ext_int(const icicle::ConfigExtension* ext, const char* key, int dflt)
   {
     // unknown keys must be tolerated (the tests set CUDA-backend keys unconditionally); has() never throws

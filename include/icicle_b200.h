@@ -391,6 +391,64 @@ B200_API int b200_merkle_tree_get_proofs(b200_merkle_tree_handle tree, const voi
                                          void* leaf_out, void* path_out);
 B200_API int b200_merkle_tree_destroy(b200_merkle_tree_handle tree);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * General-purpose hashes -- replace the Keccak / SHA3 / Blake2s / Blake3 factory hooks (REGISTER_KECCAK_256/KECCAK_512/
+ * SHA3_256/SHA3_512_FACTORY_BACKEND, icicle/include/icicle/backend/hash/keccak_backend.h; REGISTER_BLAKE2S_FACTORY_BACKEND,
+ * blake2s_backend.h; REGISTER_BLAKE3_FACTORY_BACKEND, blake3_backend.h; frontends icicle/src/hash/keccak.cpp, blake2s.cpp,
+ * blake3.cpp) and the HashBackend::hash they return, i.e. KeccakBackendCPU (icicle/backend/cpu/src/hash/cpu_keccak.cpp),
+ * Blake2sBackendCPU (cpu_blake2s.cpp) and Blake3BackendCPU (cpu_blake3.cpp), byte for byte.
+ * ---------------------------------------------------------------------------------------------------------------- */
+enum {
+  B200_HASH_KECCAK_256 = 0, /* 32-byte digest, rate 136, padding 0x01 .. 0x80 */
+  B200_HASH_KECCAK_512 = 1, /* 64-byte digest, rate 72 */
+  B200_HASH_SHA3_256 = 2,   /* FIPS 202: as Keccak-256 with padding 0x06 .. 0x80 */
+  B200_HASH_SHA3_512 = 3,
+  B200_HASH_BLAKE2S = 4,    /* unkeyed BLAKE2s-256 */
+  B200_HASH_BLAKE3 = 5      /* BLAKE3 hash mode, 32-byte digest; rows over 1024 bytes run the chunk tree */
+};
+typedef struct b200_hasher* b200_hasher_handle;
+
+/* a host object (it works on whichever device is current); input_chunk_size is the default row size of hash() and the
+ * Merkle-layer chunk (0: none).  INVALID_ARGUMENT for an unknown kind. */
+B200_API int b200_hasher_create(int kind, uint64_t input_chunk_size, b200_hasher_handle* handle);
+/* cfg->batch rows of size_bytes each (0: the default chunk), read contiguously from host or device memory at any alignment,
+ * into batch digests.  INVALID_ARGUMENT when both sizes are 0 (the reference asserts, hash_backend.h:69-75); batch 0 does
+ * nothing.  Host outputs, or is_async == 0, synchronise cfg->stream. */
+B200_API int b200_hasher_hash(b200_hasher_handle handle, const void* input, uint64_t size_bytes, const b200_hash_config* cfg,
+                              void* output);
+B200_API int b200_hasher_output_size(b200_hasher_handle handle, uint64_t* bytes);
+B200_API int b200_hasher_destroy(b200_hasher_handle handle);
+/* the Merkle-layer descriptor of a hasher: chunk = its input_chunk_size, output = its digest; the handle must outlive every
+ * tree (or PoW call) that uses the descriptor */
+B200_API int b200_hasher_merkle_layer(b200_hasher_handle handle, b200_merkle_layer* out);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * Proof of work -- replaces the PowSolverImpl / PowVerifyImpl hooks (REGISTER_POW_SOLVER_BACKEND /
+ * REGISTER_POW_VERIFY_BACKEND, icicle/include/icicle/backend/hash/pow_backend.h; frontend icicle/src/hash/pow.cpp), i.e.
+ * cpu_pow / cpu_pow_verify (icicle/backend/cpu/src/hash/cpu_pow.cpp:63-164).  The hash is any layer descriptor
+ * (b200_hasher_merkle_layer, b200_poseidon2_merkle_layer, ...).  A row is challenge || nonce (LE u64) || padding_size zero
+ * bytes; mined_hash is the first 8 digest bytes read as a LE u64; a nonce solves when mined_hash < 2^(64 - bits).
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* mirror of icicle::PowConfig (icicle/include/icicle/hash/pow.h:16-25); `ext` has no counterpart */
+typedef struct {
+  void* stream;
+  uint8_t is_challenge_on_device;
+  uint8_t is_async;            /* accepted and ignored: the solver and the verifier return with their outputs written */
+  uint8_t reserved[2];
+  uint32_t padding_size;       /* default 24 */
+} b200_pow_config;
+
+B200_API void b200_pow_default_config(b200_pow_config* cfg); /* default_pow_config(): padding 24, challenge on host */
+/* The smallest nonce that solves, as the reference's in-order scan finds it: host-driven batches of increasing nonces, each
+ * one bounded launch to write the nonces, one batched call of hash->hash and one bounded launch that takes the smallest
+ * hit; *found = 0 only when no nonce below 2^64 solves.  INVALID_ARGUMENT for bits outside 1..60 (cpu_pow.cpp:74-77) or a
+ * hash whose output is shorter than 8 bytes (the reference reads past such digests). */
+B200_API int b200_pow_solve(const b200_merkle_layer* hash, const void* challenge, uint32_t challenge_size, uint8_t bits,
+                            const b200_pow_config* cfg, int* found, uint64_t* nonce, uint64_t* mined_hash);
+/* one row for `nonce`: *is_correct = mined_hash < 2^(64 - bits); same argument checks as the solver */
+B200_API int b200_pow_verify(const b200_merkle_layer* hash, const void* challenge, uint32_t challenge_size, uint8_t bits,
+                             const b200_pow_config* cfg, uint64_t nonce, int* is_correct, uint64_t* mined_hash);
+
 /* slice (cpu_vec_ops.cpp:577-596): out[i] = in[offset + i*stride] */
 B200_API int b200_slice(int field, const void* in, uint64_t offset, uint64_t stride, uint64_t size_in, uint64_t size_out,
                const b200_vec_ops_config* cfg, void* out);
