@@ -12,7 +12,7 @@ import enum
 import numpy as np
 
 from . import capi
-from .capi import IcicleError, HashConfigC, MatMulConfigC, MerkleConfigC, MerkleLayerC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, PowConfigC, VecOpsConfigC, lib, check
+from .capi import IcicleError, FriConfigC, HashConfigC, MatMulConfigC, MerkleConfigC, MerkleLayerC, MsmConfigC, NttConfigC, Poseidon2ConstantsC, PowConfigC, VecOpsConfigC, lib, check
 
 
 class Field(enum.IntEnum):
@@ -1046,6 +1046,27 @@ class MerkleTree:
             self.close()
         except Exception:
             pass
+
+
+# ---- FRI ------------------------------------------------------------------------------------------------------------------
+def fri_fold(field, evals, n, alpha, output=None, stream=None, is_async=False, output_on_device=None):
+    """One FRI fold (b200_fri_fold): out[i] = (e[i] + e[i+n/2])/2 + alpha * (e[i] - e[i+n/2])/2 * w_n^-i over the NTT domain
+    of `field`'s base field.  `evals`: n elements (numpy or torch, host or device); `alpha`: one element on the host;
+    returns n/2 elements, on the device when `evals` is (or as `output` / `output_on_device` say).  `output` may be
+    `evals` itself: the fold is then written over its first half."""
+    ep, e_dev, _ke = _ptr(evals)
+    al = np.ascontiguousarray(alpha, dtype=np.uint32).reshape(-1)
+    if al.size != field_limbs(field):
+        raise ValueError("alpha must be one element of the field")
+    if output is None:
+        output = _out_like(field, int(n) // 2, e_dev if output_on_device is None else output_on_device)
+    op, o_dev, _ko = _out_ptr(output)
+    c = FriConfigC()
+    lib.b200_fri_default_config(C.byref(c))
+    c.stream = _stream_handle(stream)
+    c.is_input_on_device, c.is_output_on_device, c.is_async = int(e_dev), int(o_dev), int(bool(is_async))
+    check(lib.b200_fri_fold(int(field), ep, int(n), al.ctypes.data, C.byref(c), op), "fri_fold")
+    return output
 
 
 def slice(field, a, offset, stride, size_in, size_out, config=None, output=None):

@@ -90,6 +90,13 @@ class PowConfigC(C.Structure):
     ]
 
 
+class FriConfigC(C.Structure):
+    _fields_ = [
+        ("stream", C.c_void_p), ("is_input_on_device", C.c_uint8), ("is_output_on_device", C.c_uint8), ("is_async", C.c_uint8),
+        ("reserved", C.c_uint8 * 5),
+    ]
+
+
 # every symbol include/icicle_b200.h declares: name -> (restype, argtypes)
 _vp, _i, _u64, _u32, _sz = C.c_void_p, C.c_int, C.c_uint64, C.c_uint32, C.c_size_t
 SYMBOLS = {
@@ -110,6 +117,7 @@ SYMBOLS = {
     "b200_destroy_stream": (_i, [_vp]),
     "b200_host_alloc_pinned": (_i, [C.POINTER(_vp), _sz]),
     "b200_host_free_pinned": (_i, [_vp]),
+    "b200_pointer_is_on_device": (_i, [_vp, C.POINTER(_i)]),
     "b200_field_bytes": (_i, [_i]),
     "b200_curve_scalar_field": (_i, [_i]),
     "b200_curve_affine_bytes": (_i, [_i]),
@@ -166,6 +174,8 @@ SYMBOLS = {
                             C.POINTER(_u64), C.POINTER(_u64)]),
     "b200_pow_verify": (_i, [C.POINTER(MerkleLayerC), _vp, _u32, C.c_uint8, C.POINTER(PowConfigC), _u64, C.POINTER(_i),
                              C.POINTER(_u64)]),
+    "b200_fri_default_config": (None, [C.POINTER(FriConfigC)]),
+    "b200_fri_fold": (_i, [_i, _vp, _u64, _vp, C.POINTER(FriConfigC), _vp]),
     "b200_slice": (_i, [_i, _vp, _u64, _u64, _u64, _u64, C.POINTER(VecOpsConfigC), _vp]),
     "b200_affine_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),
     "b200_projective_convert_montgomery": (_i, [_i, _vp, _u64, _i, C.POINTER(VecOpsConfigC), _vp]),

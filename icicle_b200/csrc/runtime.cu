@@ -301,6 +301,13 @@ int b200_host_free_pinned(void* ptr)
   return B200_SUCCESS;
 }
 
+int b200_pointer_is_on_device(const void* ptr, int* on_device)
+{
+  if (!ptr || !on_device) return B200_INVALID_POINTER;
+  *on_device = ptr_on_device(ptr, false) ? 1 : 0;
+  return B200_SUCCESS;
+}
+
 int b200_field_bytes(int field) { return 4 * field_limbs(field); }
 
 int b200_curve_scalar_field(int curve)

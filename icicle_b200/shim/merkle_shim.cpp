@@ -60,14 +60,19 @@ namespace {
     eIcicleError build(const std::byte* leaves, uint64_t leaves_size, const MerkleTreeConfig& config) override
     {
       const b200_merkle_config c = to_c(config);
+      m_root_host_valid = false;
       return to_err(b200_merkle_tree_build(m_tree, leaves, leaves_size, &c));
     }
 
-    // a host copy; waits for an async build's stream (b200_merkle_tree_get_root)
+    // a host copy; waits for an async build's stream (b200_merkle_tree_get_root).  Read from the device once per build:
+    // every proof carries the root, and a FRI prover asks for hundreds of proofs of one tree
     std::pair<const std::byte*, size_t> get_merkle_root() const override
     {
-      m_root_host.resize(m_root_size);
-      if (b200_merkle_tree_get_root(m_tree, m_root_host.data(), 0)) return {nullptr, 0};
+      if (!m_root_host_valid) {
+        m_root_host.resize(m_root_size);
+        if (b200_merkle_tree_get_root(m_tree, m_root_host.data(), 0)) return {nullptr, 0};
+        m_root_host_valid = true;
+      }
       return {m_root_host.data(), m_root_host.size()};
     }
 
@@ -106,6 +111,7 @@ namespace {
     b200_merkle_tree_handle m_tree = nullptr;
     uint64_t m_root_size = 0;
     mutable std::vector<std::byte> m_root_host;
+    mutable bool m_root_host_valid = false; // m_root_host holds the root of the last build
     mutable void* m_root_dev = nullptr;
   };
 

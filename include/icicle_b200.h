@@ -106,6 +106,9 @@ B200_API int b200_destroy_stream(void* stream);                    /* DeviceAPI:
 /* pinned host staging (used by the e2e path and by bench.py; not part of the reference API) */
 B200_API int b200_host_alloc_pinned(void** ptr, size_t bytes);
 B200_API int b200_host_free_pinned(void* ptr);
+/* *on_device = 1 when the driver knows `ptr` as device or managed memory, 0 for anything else (pageable or pinned host memory):
+ * what b200_fri_fold and the FRI registration check their placement flags against */
+B200_API int b200_pointer_is_on_device(const void* ptr, int* on_device);
 /* size in bytes of one element of `field` / one affine or projective point of `curve` */
 B200_API int b200_field_bytes(int field);
 B200_API int b200_curve_scalar_field(int curve);
@@ -448,6 +451,33 @@ B200_API int b200_pow_solve(const b200_merkle_layer* hash, const void* challenge
 /* one row for `nonce`: *is_correct = mined_hash < 2^(64 - bits); same argument checks as the solver */
 B200_API int b200_pow_verify(const b200_merkle_layer* hash, const void* challenge, uint32_t challenge_size, uint8_t bits,
                              const b200_pow_config* cfg, uint64_t nonce, int* is_correct, uint64_t* mined_hash);
+
+/* ------------------------------------------------------------------------------------------------------------------
+ * FRI fold -- the arithmetic of one commit-phase round of the FRI prover (FriBackend::get_proof,
+ * icicle/include/icicle/backend/fri_backend.h; CpuFriBackend::commit_fold_phase, icicle/backend/cpu/include/
+ * cpu_fri_backend.h:113-132).  The prover itself (trees, transcript, PoW, queries) is the registration shim
+ * icicle_b200/shim/fri_shim.cpp over this entry point and the Merkle / hash / PoW ones above.
+ * ---------------------------------------------------------------------------------------------------------------- */
+/* in the style of b200_vec_ops_config.  A pointer's placement is asked of the driver: a device pointer is used in place
+ * whatever its flag says, and a flag that claims device memory for a pointer that is not is INVALID_ARGUMENT. */
+typedef struct {
+  void* stream;
+  uint8_t is_input_on_device;
+  uint8_t is_output_on_device;
+  uint8_t is_async;            /* honoured when the output is on the device; a host output is complete on return */
+  uint8_t reserved[5];
+} b200_fri_config;
+
+B200_API void b200_fri_default_config(b200_fri_config* cfg); /* null stream, host input and output, synchronous */
+/* out[i] = (in[i] + in[i + n/2]) / 2 + alpha * (in[i] - in[i + n/2]) / 2 * w^-i for i < n/2, where w is the n-th root of
+ * unity of the NTT domain (b200_ntt_init_domain) of `field`'s base field.  `field` is a base field with an NTT, or
+ * B200_FIELD_*_EXT4 / B200_FIELD_GOLDILOCKS_EXT2: in, out and alpha are then extension elements, the twiddles stay in the
+ * base field.  in: n elements; out: n/2 elements; alpha: one element on the host; all canonical standard form.
+ * out == in (the fold written over the first half of its input) is supported; any other overlap of the two ranges is
+ * INVALID_ARGUMENT.  INVALID_ARGUMENT also for n < 2 or not a power of two, no initialised domain on the current device or
+ * n above its size, and a non-canonical alpha; API_NOT_IMPLEMENTED for a field without an NTT.  All of these are checked
+ * on the host before anything is launched. */
+B200_API int b200_fri_fold(int field, const void* in, uint64_t n, const void* alpha, const b200_fri_config* cfg, void* out);
 
 /* slice (cpu_vec_ops.cpp:577-596): out[i] = in[offset + i*stride] */
 B200_API int b200_slice(int field, const void* in, uint64_t offset, uint64_t stride, uint64_t size_in, uint64_t size_out,
